@@ -159,8 +159,9 @@ void md_debug_set_pdl(int enable);
  * bit0 [qkv;fc1] GEMM, bit1 its epilogue, bit2 attention, bit3 [proj|fc2] GEMM, bit4 residual+LN epilogue. */
 void md_debug_skip_decode_kernels(int mask);
 /* Timing experiments only: bit5 stops the row-form GEMM from releasing its dependent grid early (programmatic dependent
- * launch); bit7 runs the patch embedding as patchify kernel + row-form GEMM instead of the im2col-fused kernel.  Other
- * bits are ignored. */
+ * launch); bit7 runs the patch embedding as patchify kernel + row-form GEMM instead of the im2col-fused kernel; bit8
+ * makes the row-form GEMM use 128-wide column tiles for every N >= 96 instead of the planned 192 / 256 (same results,
+ * for A/B timing and tests).  Other bits are ignored. */
 void md_debug_gemm(int flags);
 /* Experiments only: cap the persistent row-form GEMM's grid at `sms` SMs (0 = all, the default), leaving the others
  * to kernels of a concurrent stream (encode / decode overlap experiments). */

@@ -7,6 +7,11 @@
 //   warpgroups 1, 2 : consumers     (wgmma m64 x BN x 16 from shared memory, accumulators in registers, then the
 //                                    fused epilogue straight from the registers)
 //
+// Row form: BN = 256 / 192 for the wide layers (per k16 step a warpgroup reads 64 x 16 of A and BN x 16 of B from
+// shared memory, so a wider tile needs fewer shared-memory bytes per MMA), with the producer warpgroup's registers
+// handed to the consumers (setmaxnreg) for the 128 / 96 accumulators per thread.  The consumers keep one k-block of
+// MMAs in flight while they wait for the next stage; each accumulator still sums K in the order its MMAs are issued.
+//
 // Tails in M, N and K are handled by TMA out-of-bounds zero fill plus masked stores, so the awkward reference
 // shapes (K=588->592, N=4304, M=B*729) need no padded copies of activations.
 //
@@ -114,7 +119,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const GemmParams p) {
   using S = GemmSmem<BN, STAGES>;
-  static_assert(BN == 32 || BN == 64 || BN == 128, "BN");
+  static_assert(BN == 32 || BN == 64 || BN == 128 || BN == 192 || BN == 256, "BN");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
@@ -141,8 +146,11 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int total_tiles = p.m_blocks * p.n_blocks;
   const int wg = threadIdx.x >> 7;
 
+  // 384 threads launch with 168 registers each; 40 x 128 + 232 x 256 <= 65536 moves the producer's share to the
+  // consumers' accumulators
   if (wg == 0) {
     // ------------------------------ TMA producer ------------------------------
+    setmaxnreg_dec<40>();
     if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -163,6 +171,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     }
   } else {
     // ------------------------------ consumers: MMA + epilogue ------------------------------
+    setmaxnreg_inc<232>();
     const int c = wg - 1;                      // accumulator rows 64c .. 64c+63 of the tile
     const int t = threadIdx.x & 127;
     const int lane = t & 31, w = t >> 5, qd = lane & 3;
@@ -176,6 +185,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       float acc[BN / 2];
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      int prev = -1;                           // stage whose MMAs are still in flight
       for (int kb = 0; kb < p.k_blocks; ++kb) {
         mbar_wait(&full_bar[stage], phase);
         if (tl && first && t == 0 && c == 0) tl_s[2] = tl_now();      // first operands landed
@@ -190,11 +200,15 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           wgmma_ss<BN>(acc, da + static_cast<uint64_t>(2 * k), db + static_cast<uint64_t>(2 * k),
                        (kb > 0 || k > 0) ? 1u : 0u);
         wgmma_commit();
-        wgmma_wait<0>();
+        wgmma_wait<1>();                       // k-block kb - 1 is done: its operands may be overwritten
         fence_regs(acc);
-        if (t == 0) mbar_arrive(&empty_bar[stage]);
+        if (t == 0 && prev >= 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
+      wgmma_wait<0>();
+      fence_regs(acc);
+      if (t == 0) mbar_arrive(&empty_bar[prev]);
       if (tl && t == 0 && c == 0) tl_s[3] = tl_now();                   // (last) accumulator complete
 
 #pragma unroll
@@ -638,7 +652,9 @@ int timeline_install_all(unsigned long long* buf, unsigned int* count, unsigned 
 
 static int dispatch_gemm(int bn, const CUtensorMap& tA, const CUtensorMap& tB, const GemmParams& p,
                          cudaStream_t stream) {
-  switch (bn) {
+  switch (bn) {      // stage = 16 KB of A + BN x 128 B of B; one stage is held by the MMAs in flight
+    case 256: return launch_gemm<256, 4>(tA, tB, p, stream);
+    case 192: return launch_gemm<192, 5>(tA, tB, p, stream);
     case 128: return launch_gemm<128, 6>(tA, tB, p, stream);
     case 64: return launch_gemm<64, 8>(tA, tB, p, stream);
     case 32: return launch_gemm<32, 10>(tA, tB, p, stream);
@@ -646,12 +662,15 @@ static int dispatch_gemm(int bn, const CUtensorMap& tA, const CUtensorMap& tB, c
   return set_error("unsupported BN");
 }
 
-// 128-wide tiles give the tensor pipe the longest uninterrupted run (64 accumulator registers per thread); fall
-// back for narrow N.
+// Row-form tile width: the widest of 256 / 192 / 128 whose padding of the last column tile costs at most 5 % of N
+// (256 for N = 2048, 3456, 4304, 6144, 8192; 192 for N = 1152), 64 / 32 for narrow N.  md_debug_gemm bit 8 keeps
+// every wide N at 128 (A/B timing and tests).
 static int pick_bn_rows(int N) {
-  if (N >= 96) return 128;
-  if (N >= 48) return 64;
-  return 32;
+  if (N < 96) return N >= 48 ? 64 : 32;
+  if (!(g_gemm_debug & 256))
+    for (int bn : {256, 192})
+      if (static_cast<long long>((N + bn - 1) / bn * bn - N) * 20 <= N) return bn;
+  return 128;
 }
 
 static int run_rowform(const CUtensorMap& tA, const CUtensorMap& tB, int bn, GemmParams& p, cudaStream_t stream) {
@@ -698,7 +717,7 @@ int gemm_rowform_qkv_rope(const __nv_bfloat16* A, long long lda, const __nv_bflo
   if (M <= 0 || K <= 0) return set_error("gemm_qkv_rope: empty problem");
   if (K % 8 || epi.D % 64 || epi.D != epi.n_heads * 64 || epi.n_kv_heads <= 0 || epi.n_heads % epi.n_kv_heads || !bias)
     return set_error("gemm_qkv_rope: unsupported shape");
-  const int bn = 128;                                // 2 heads per column tile; N is a multiple of 64
+  const int bn = pick_bn_rows(N);                    // 2 to 4 heads per column tile: N and BN are multiples of 64
   CUtensorMap tA, tB;
   if (make_tmap_bf16_2d(&tA, A, M, K, lda, BM)) return 1;
   if (make_tmap_bf16_2d(&tB, W, N, K, ldw, bn)) return 1;

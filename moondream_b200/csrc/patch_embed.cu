@@ -12,7 +12,8 @@
 //                     chunk run wgmma m64 x 128 x 16 on their 64 rows and drain the registers: + bias, round, + pos_emb,
 //                     round, stores
 // Persistent over row tiles (one CTA per SM).  The accumulation order over K is the row-form GEMM's (the same K = 16
-// MMAs in the same order), so the result equals patchify + gemm_rowform bit for bit (tests/test_kernels_gpu.py).
+// steps in the same order; the row form's wider n192 / n256 instruction gives the same bits per element), so the result
+// equals patchify + gemm_rowform bit for bit (tests/test_model_parity_gpu.py).
 #include "kernels.cuh"
 #include "ptx.cuh"
 
