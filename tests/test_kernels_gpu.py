@@ -34,20 +34,23 @@ def test_layernorm(rows, dim):
     assert ((y != ref).float().mean().item()) < 0.02
 
 
-@pytest.mark.parametrize("impl", [0, 1, 2, 4], ids=["tcgen05_single_pass", "mma_sync", "tcgen05_two_pass", "tcgen05_single_pass_one_item_per_cta"])
-@pytest.mark.parametrize("n_crops,heads", [(1, 16), (3, 2), (2, 10)])
+@pytest.mark.parametrize("impl", [0, 1, 4], ids=["wgmma_persistent", "mma_sync", "wgmma_one_item_per_cta"])
+@pytest.mark.parametrize("n_crops,heads", [(1, 16), (3, 2), (2, 10), (5, 16)])
 def test_vit_attention(n_crops, heads, impl):
     N, lib = _lib()
-    lib.md_debug_attention_impl(impl)
     seq, hd = 729, 72
     D = heads * hd
     g = torch.Generator(device="cuda").manual_seed(n_crops * 10 + heads)
     qkv = torch.randn(n_crops * seq, 3 * D, device="cuda", generator=g).bfloat16()
     out = torch.empty(n_crops * seq, D, device="cuda", dtype=torch.bfloat16)
-    N.check(lib.md_vit_attention_bf16(N.ptr(qkv), n_crops, seq, heads, N.ptr(out), N.current_stream()))
+    lib.md_debug_attention_impl(impl)
+    try:
+        N.check(lib.md_vit_attention_bf16(N.ptr(qkv), n_crops, seq, heads, N.ptr(out), N.current_stream()))
+        torch.cuda.synchronize()
+    finally:
+        lib.md_debug_attention_impl(0)
     q, k, v = [t.view(n_crops, seq, heads, hd).transpose(1, 2).float() for t in qkv.chunk(3, dim=-1)]
     ref = F.scaled_dot_product_attention(q, k, v).transpose(1, 2).reshape(n_crops * seq, D)
-    lib.md_debug_attention_impl(0)
     assert rel(out, ref) < 6e-3, rel(out, ref)
 
 
@@ -75,12 +78,21 @@ def _rope_ref(x, table, pos):
     return torch.cat([rot, x[..., 32:]], dim=-1)
 
 
-@pytest.mark.parametrize("impl", [0, 1, 2, 4], ids=["tcgen05_single_pass", "mma_sync", "tcgen05_two_pass", "tcgen05_single_pass_one_item_per_cta"])
-def test_rope_prefill_decode_attention(impl):
+@pytest.mark.parametrize("layer", [0, 1])
+@pytest.mark.parametrize("impl", [0, 1, 4], ids=["wgmma_persistent", "mma_sync", "wgmma_one_item_per_cta"])
+def test_rope_prefill_decode_attention(impl, layer):
+    N, lib = _lib()
+    lib.md_debug_attention_impl(impl)
+    try:
+        _rope_prefill_decode_attention(layer)
+    finally:
+        lib.md_debug_attention_impl(0)
+
+
+def _rope_prefill_decode_attention(layer):
     from moondream_b200.engine import rope_table
 
     N, lib = _lib()
-    lib.md_debug_attention_impl(impl)
     heads, layers, n_pages, max_blocks, prefix = 4, 2, 64, 16, 730
     D = heads * 64
     lens = [730, 730, 17]
@@ -91,7 +103,6 @@ def test_rope_prefill_decode_attention(impl):
     kv = N.md_kv(pool=pool.data_ptr(), n_pages=n_pages, block_tables=bt.data_ptr(), max_blocks=max_blocks,
                  n_layers=layers)
     g = torch.Generator(device="cuda").manual_seed(3)
-    layer = 1
     # sequence 2 needs its prefix (positions 0..729) in the cache first: run a 730-token prefill for it
     for (lens_i, starts_i) in (([730, 730, 730], [0, 0, 0]), (lens, starts)):
         T = sum(lens_i)
@@ -140,7 +151,6 @@ def test_rope_prefill_decode_attention(impl):
         q = q_out[s].float().view(heads, 1, 64)
         ref = F.scaled_dot_product_attention(q, kc, vc).reshape(D)
         assert rel(out[s], ref) < 6e-3, (s, rel(out[s], ref))
-    lib.md_debug_attention_impl(0)
 
 
 @pytest.mark.parametrize("vocab", [2048, 16384])
