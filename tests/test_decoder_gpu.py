@@ -251,18 +251,25 @@ def _check_against_reference(got, rounded, truth, what):
 
 
 # ------------------------------------------------------------------------------------------------ models
-@pytest.fixture(scope="module")
-def model(request):
-    """Engine over the tiny vision tower and a two-layer decoder of the given shape, plus its fp64 reference"""
-    from moondream_b200 import config as C, synth
-    from moondream_b200.engine import Engine
+def _config(shape):
+    """the tiny vision tower in front of a two-layer decoder of shape (dim, heads, kv heads, ff)"""
+    from moondream_b200 import config as C
 
-    dim, heads, kvh, ff = SHAPES[request.param]
+    dim, heads, kvh, ff = shape
     cfg = C.tiny()
-    cfg = dataclasses.replace(
+    return dataclasses.replace(
         cfg, text=dataclasses.replace(cfg.text, dim=dim, n_heads=heads, n_kv_heads=kvh, ff_dim=ff, n_layers=2,
                                       vocab_size=2048),
         vision=dataclasses.replace(cfg.vision, proj_out_dim=dim), region=dataclasses.replace(cfg.region, dim=dim))
+
+
+@pytest.fixture(scope="module")
+def model(request):
+    """Engine over the tiny vision tower and a two-layer decoder of the given shape, plus its fp64 reference"""
+    from moondream_b200 import synth
+    from moondream_b200.engine import Engine
+
+    cfg = _config(SHAPES[request.param])
     sd = synth.synthetic_state_dict(cfg, 5)
     eng = Engine(cfg, sd, max_batch=1, kv_pages=1)          # the tests bring their own KV pools
     ref = _Ref(cfg, sd)

@@ -12,10 +12,43 @@ import torch
 pytestmark = pytest.mark.gpu
 
 
+# per-group scale exponents, cycled so that neighbouring groups differ by orders of magnitude; 2^-133 makes the
+# scale itself and every product with it fp32-subnormal
+EDGE_EXPONENTS = (-20, 4, -7, 0, -133, 2, -14)
+
+
+def _edges(bits, n_out, K, g):
+    """A QuantLinear built directly: int8 bytes over the whole range (-128, -127, 0, 127 at the start of each row), int4
+    nibbles 0 and 15 in both halves of a byte, per-group scales 2^e * (1 + u) with e from EDGE_EXPONENTS, and for int4
+    fractional zero points in [0, 16), every other group's bf16-valued (a reference checkpoint stores zero_point as
+    bf16; the stream layout holds fp32)."""
+    from moondream_b200 import quant
+
+    groups = K // 128
+    if bits == 4:
+        q = torch.randint(0, 16, (n_out, K), generator=g, dtype=torch.uint8)
+        q[:, :8] = torch.tensor([0, 15, 15, 0, 0, 0, 15, 15], dtype=torch.uint8)     # bytes 0xf0, 0x0f, 0x00, 0xff
+        zero = torch.rand(n_out, groups, generator=g) * 16
+        zero[:, 1::2] = zero[:, 1::2].bfloat16().float()
+    else:
+        q = torch.randint(0, 256, (n_out, K), generator=g, dtype=torch.uint8)
+        q[:, :4] = torch.tensor([128, 129, 0, 127], dtype=torch.uint8)                 # -128, -127, 0, 127
+        zero = torch.zeros(n_out, groups)                                              # the int8 layout's zero point
+    e = torch.tensor(EDGE_EXPONENTS, dtype=torch.float64)
+    idx = (torch.arange(n_out).view(-1, 1) + torch.arange(groups).view(1, -1)) % len(EDGE_EXPONENTS)
+    scale = (2.0 ** e[idx] * (1 + torch.rand(n_out, groups, generator=g, dtype=torch.float64))).float()
+    return quant.QuantLinear(bits, q, scale.contiguous(), zero.contiguous())
+
+
 def _packed(bits, n_out, K, seed, awkward=False):
+    """(QuantLinear, its dequantised bf16 matrix).  awkward: False = quantised from a random matrix; True = int4
+    scales perturbed off bf16 and fractional zero points; "edges" = _edges."""
     from moondream_b200 import quant
 
     g = torch.Generator().manual_seed(seed)
+    if awkward == "edges":
+        ql = _edges(bits, n_out, K, g)
+        return ql, ql.dequantized()
     w = (torch.randn(n_out, K, generator=g) / K ** 0.5).to(torch.bfloat16)
     if bits == 4:
         nib, scale, zero = quant.quantize_weight_int4(w)
@@ -32,7 +65,10 @@ def _packed(bits, n_out, K, seed, awkward=False):
 
 
 @pytest.mark.parametrize("bits", [4, 8])
-@pytest.mark.parametrize("n_out,K,awkward", [(64, 128, False), (100, 256, True), (640, 1024, True), (2048, 2048, False)])
+@pytest.mark.parametrize("n_out,K,awkward", [
+    (64, 128, False), (100, 256, True), (640, 1024, True), (2048, 2048, False),
+    (14336, 2048, True), (2048, 10240, True),                     # the 2B decoder's W1 = [qkv ; fc1], W2 = [proj | fc2]
+    (100, 256, "edges"), (14336, 2048, "edges"), (2048, 10240, "edges")])
 def test_dequantize_kernel_is_bit_exact(bits, n_out, K, awkward):
     from moondream_b200 import ops
 
@@ -46,7 +82,46 @@ def test_dequantize_kernel_is_bit_exact(bits, n_out, K, awkward):
 
 
 STREAM_SHAPES = [  # (batch, n_out, K): 2B [qkv;fc1], fc2-like, 0.5B [qkv;fc1] at b128, ragged batch / rows, tiny
-    (32, 14336, 2048), (32, 2048, 8192), (128, 7168, 1024), (70, 1000, 512), (5, 640, 128), (64, 4096, 256)]
+    (32, 14336, 2048), (32, 2048, 8192), (128, 7168, 1024), (70, 1000, 512), (5, 640, 128), (64, 4096, 256),
+    # GQA-4 [qkv;fc1] (splits of 11 k-blocks start on odd k-blocks), 0.5B [qkv;fc1] past one 128-row launch, and two
+    # more plans with odd split starts at multi-k-block splits
+    (32, 11264, 2048), (130, 11264, 2048), (129, 7168, 1024), (256, 7168, 1024), (32, 3072, 4096), (16, 7168, 10240)]
+
+
+def _plan_smallbatch(n_out, K, sms):
+    """gemm.cu plan_smallbatch (kb_divisor 0): (tile rows, k-blocks per split, splits)"""
+    k_blocks = -(-K // 64)
+    best, best_cost = (128, k_blocks, 1), None
+    for kb in range(k_blocks, 0, -1):
+        splits = -(-k_blocks // kb)
+        if splits > 32 or (kb < 4 and k_blocks >= 4):
+            break
+        for rows in (128, 64):
+            waves = -(-(-(-n_out // rows) * splits) // sms)
+            cost = waves * rows * kb + splits * n_out * 32 * 8 // (128 * sms)
+            if best_cost is None or cost < best_cost:
+                best, best_cost = (rows, kb, splits), cost
+    return best
+
+
+def test_stream_shapes_reach_odd_split_starts():
+    """A split that starts on an odd k-block and spans more than one k-block reads the quantisation groups at an
+    offset (gl = ((kb0 + j) >> 1) - g0 in smallbatch_gemm_kernel).  Whether STREAM_SHAPES reach that case depends on
+    the SM count, so the plan is restated here, checked against the library's split count, and the case required."""
+    from moondream_b200 import _native as N
+
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    odd = []
+    for n_out, K in dict.fromkeys((n_out, K) for _, n_out, K in STREAM_SHAPES):
+        _, kb, splits = _plan_smallbatch(n_out, K, sms)
+        got = N.lib().md_linear_small_batch_splits(n_out, K)
+        assert got == splits, f"({n_out}, {K}) on {sms} SMs: the library plans {got} splits, the restated " \
+                              f"plan_smallbatch {splits}; update _plan_smallbatch"
+        if any(s * kb % 2 and min(kb, -(-K // 64) - s * kb) > 1 for s in range(splits)):
+            odd.append((n_out, K))
+    assert odd, f"on this device ({sms} SMs) no STREAM_SHAPES entry has a split starting on an odd k-block with more " \
+                f"than one k-block: add a shape that does"
+    print(f"{sms} SMs: odd split starts with > 1 k-block at {odd}")
 
 
 @pytest.mark.parametrize("bits", [4, 8])
@@ -54,7 +129,7 @@ STREAM_SHAPES = [  # (batch, n_out, K): 2B [qkv;fc1], fc2-like, 0.5B [qkv;fc1] a
 def test_quantised_stream_equals_bf16_stream_on_dequantised_weights(bits, batch, n_out, K):
     from moondream_b200 import ops
 
-    ql, w = _packed(bits, n_out, K, batch + n_out + K + bits, awkward=(bits == 4))
+    ql, w = _packed(bits, n_out, K, batch + n_out + K + bits, awkward="edges")
     g = torch.Generator(device="cuda").manual_seed(batch + K)
     x = torch.randn(batch, K, device="cuda", generator=g).bfloat16()
     b = torch.randn(n_out, device="cuda", generator=g).bfloat16()
