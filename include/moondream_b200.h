@@ -151,7 +151,10 @@ int md_prefill_attention_bf16(const void* q, int n_heads, int total_tokens, cons
                               const int* start_pos, int n_seqs, int max_q, int prefix_len,
                               const md_kv* kv, int layer, void* out, void* stream);
 /* Testing / A-B timing only: 1 = the legacy mma.sync kernels, 4 = the wgmma kernels launched with one CTA per work item
- * instead of persistent CTAs; any other value = the wgmma kernels with persistent CTAs (the default). */
+ * instead of persistent CTAs; any other value = the wgmma kernels with persistent CTAs (the default).
+ * Decode attention (md_decode_attention_bf16 and the decode step): 2 = the kernel that loads K/V into registers instead
+ * of the one streaming them through a bulk-copy ring (the same bits).  Prefill and ViT attention treat 2 as the
+ * default. */
 void md_debug_attention_impl(int impl);
 /* Testing / A-B timing only: programmatic dependent launch between consecutive kernels (default on). */
 void md_debug_set_pdl(int enable);

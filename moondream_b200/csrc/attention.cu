@@ -9,9 +9,10 @@
 //        prefix-LM mask computed from indices (positions < prefix attend bidirectionally inside the
 //        prefix, causal afterwards); K/V come from the paged KV pool and only the pos+T keys that
 //        exist are visited (the reference scans all 2048 cache slots under a bool mask).
-//  * decode_attention_kernel: one query per (sequence, head), streams that head's K/V pages with
-//    coalesced 128-byte rows; HBM-bound (reference text.py:46-50 with the [1,1,2048] mask of
-//    moondream.py:472-474,514).
+//  * decode_attention_ring_kernel: one query per (sequence, head), that head's K/V pages streamed by bulk copy
+//    through a shared-memory ring; HBM-bound (reference text.py:46-50 with the [1,1,2048] mask of
+//    moondream.py:472-474,514).  decode_attention_kernel, the same computation with loads into registers, stays for
+//    A/B timing and as the tests' independent comparison.
 //
 // KV pool layout (bf16): [layer][page][2 (k,v)][head][64 tokens][64 dims]; block_tables[seq][i] is
 // the page holding positions 64*i .. 64*i+63 of that sequence.
@@ -538,7 +539,244 @@ decode_attention_kernel(const __nv_bfloat16* __restrict__ q, int n_heads, int n_
   if (tl) tl_emit((2u << 28) | (FUSED ? 1u : 0u), tl_s[0], tl_s[1], tl_s[2], tl_s[3], tl_now());
 }
 
+// ------------------------------------------------------------------------------------------------
+// decode attention with a bulk-copy ring: the same work split, lane mapping and arithmetic as decode_attention_kernel
+// (one CTA per (sequence, head); in every page warp w takes rows 16w .. 16w + 15, 4 rows per step, 8 lanes per
+// 128-byte row), so the two give the same bits.  What differs is how the K/V rows arrive: one thread streams them by
+// 1-D bulk copy into a 3-stage mbarrier ring instead of every lane loading into registers, so the bytes in flight no
+// longer depend on the compiler keeping the loads ahead of the math.  A stage is half a page in the order the warps
+// consume it: for each warp its rows 16w + 8h .. 16w + 8h + 7 of K and of V (h = 0, 1), 8 copies of 1 KB (the pool
+// keeps a (layer, page, plane, head) block contiguous).  Rows past the context arrive with the page and are left out
+// by a branch on the position, never multiplied by p = 0.
+//
+// 24 KB of ring and <= 64 registers give 8 CTAs per SM: the bench's 32 x 32 (sequence, head) pairs fit the 132 SMs in
+// one wave (the register-loading kernel fits 7 per SM, 924 at once, and streams its last 100 CTAs as a thin second
+// wave).  The following [proj | fc2] weight-stream CTA sizes its own ring to ~226 KB of shared memory and so starts on
+// SMs the attention has left, as before.
+//
+// FUSED: the new K / V row is written to the pool and also kept in shared memory, where the consumer takes it from
+// for key `pos` (selected by position).  The copies of that page are issued before the prologue computes the row and
+// may or may not see the generic-proxy global write, so their copy of the row is never used: that avoids a proxy fence
+// + block barrier in front of the first copies.
+// ------------------------------------------------------------------------------------------------
+constexpr int kDecStages = 3;
+constexpr int kDecStageElems = 2 * 4 * 8 * 64;                         // [K, V][warp][8 rows][64 dims]
+constexpr int kDecSmem = kDecStages * kDecStageElems * 2;              // 24 KB
+constexpr int kDecCtasPerSm = 8;
+
+template <bool FUSED>
+__global__ void __launch_bounds__(128, kDecCtasPerSm)
+decode_attention_ring_kernel(const __nv_bfloat16* __restrict__ q, int n_heads, int n_kv_heads, const int* __restrict__ pos,
+                             __nv_bfloat16* __restrict__ kv_pool, int n_pages,
+                             const int* __restrict__ block_tables, int max_blocks, int layer,
+                             __nv_bfloat16* __restrict__ out, long long ld_out, float scale_log2, const DecodeFuse fz) {
+  const bool tl = tl_on() && threadIdx.x == 0;
+  __shared__ unsigned long long tl_s[4];
+  if (tl) tl_s[0] = tl_now();
+  pdl_launch_dependents();
+  pdl_wait();
+  if (tl) tl_s[1] = tl_now();
+  extern __shared__ __align__(128) uint8_t dec_smem[];
+  __nv_bfloat16* ring = reinterpret_cast<__nv_bfloat16*>(dec_smem);
+  __shared__ uint64_t full_bar[kDecStages];
+  __shared__ __align__(16) __nv_bfloat16 s_new[2][64];                  // FUSED: the new K and V rows
+  __shared__ float sq[64];
+
+  const int head = blockIdx.x, seq = blockIdx.y;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int sub = lane & 7, rowi = lane >> 3;
+  const int cur = pos[seq];
+  const int kv_len = cur + 1;
+  const int n_stages = 2 * ((kv_len + kPageTokens - 1) / kPageTokens);  // two per page
+  const int* btab = block_tables + static_cast<long long>(seq) * max_blocks;
+  const int kv_head = FUSED ? head : head / (n_heads / n_kv_heads);
+  const long long head_off = static_cast<long long>(kv_head) * (kPageTokens * 64);
+  const long long v_off = static_cast<long long>(n_kv_heads) * (kPageTokens * 64);
+  const long long layer_off = static_cast<long long>(layer) * n_pages;
+
+  auto issue = [&](int k) {                              // half k & 1 of page k >> 1 into slot k % kDecStages
+    const int page = btab[k >> 1];
+    const __nv_bfloat16* src = kv_pool + (layer_off + page) * 2 * v_off + head_off + (k & 1) * 8 * 64;
+    __nv_bfloat16* dst = ring + (k % kDecStages) * kDecStageElems;
+    uint64_t* bar = &full_bar[k % kDecStages];
+    mbar_arrive_expect_tx(bar, kDecStageElems * 2);
+#pragma unroll
+    for (int pl = 0; pl < 2; ++pl)
+#pragma unroll
+      for (int w = 0; w < 4; ++w)
+        bulk_load_1d(dst + (pl * 4 + w) * 8 * 64, src + pl * v_off + w * 16 * 64, 8 * 64 * 2, bar);
+  };
+  if (tid == 0) {
+    for (int s = 0; s < kDecStages; ++s) mbar_init(&full_bar[s], 1);
+    fence_barrier_init();
+    for (int k = 0; k < kDecStages && k < n_stages; ++k) issue(k);
+  }
+
+  float qv[8];
+  if (FUSED) {
+    // the prologue of decode_attention_kernel: same features per thread, same summation order
+    const int NF = 3 * fz.D + fz.FF;
+    const long long sstride = static_cast<long long>(fz.B) * NF;
+    const float* ws0 = fz.ws + static_cast<long long>(seq) * NF;
+    const int per = fz.FF / n_heads;
+    const bool rot = warp < 2 && lane < 16;
+    const int f0 = warp * fz.D + head * 64;
+    const int fa = rot ? f0 + lane : f0 + 2 * lane;
+    const int fb = rot ? f0 + 16 + lane : f0 + 2 * lane + 1;
+    const int fh = 3 * fz.D + head * per + tid * 2;
+    const bool has_h = tid * 2 < per;
+    float ra = 0.f, rb = 0.f, ba = 0.f, bb = 0.f;
+    float2 rh = make_float2(0.f, 0.f);
+    uint32_t bh = 0;
+    if (warp < 3) {
+      ra = ws0[fa]; rb = ws0[fb];
+      ba = __bfloat162float(fz.bias[fa]); bb = __bfloat162float(fz.bias[fb]);
+    }
+    if (has_h) {
+      rh = *reinterpret_cast<const float2*>(ws0 + fh);
+      bh = *reinterpret_cast<const uint32_t*>(fz.bias + fh);
+    }
+    float cs = 0.f, sn = 0.f;
+    int new_page = 0;
+    if (rot) { cs = fz.freqs[(cur * 16 + lane) * 2]; sn = fz.freqs[(cur * 16 + lane) * 2 + 1]; }
+    if (warp == 1 || warp == 2) new_page = btab[cur >> 6];
+    auto finish = [&](float a, int f, float b) {
+#pragma unroll 1
+      for (int s2 = 1; s2 < fz.splits; ++s2) a += ws0[s2 * sstride + f];
+      return bf16_round(a + b);
+    };
+    if (has_h) {
+      const float g0 = gelu_tanh(finish(rh.x, fh, bf16_lo(bh))), g1 = gelu_tanh(finish(rh.y, fh + 1, bf16_hi(bh)));
+      *reinterpret_cast<uint32_t*>(fz.hid + seq * fz.ld_hid + head * per + tid * 2) = pack_bf16x2(g0, g1);
+    }
+    for (int i2 = tid * 2 + 256; i2 < per; i2 += 256) {
+      const int f = 3 * fz.D + head * per + i2;
+      const float g0 = gelu_tanh(finish(ws0[f], f, __bfloat162float(fz.bias[f])));
+      const float g1 = gelu_tanh(finish(ws0[f + 1], f + 1, __bfloat162float(fz.bias[f + 1])));
+      *reinterpret_cast<uint32_t*>(fz.hid + seq * fz.ld_hid + head * per + i2) = pack_bf16x2(g0, g1);
+    }
+    if (warp < 3) {                                      // warp 0: q, 1: k, 2: v of this head
+      const float va = finish(ra, fa, ba), vb = finish(rb, fb, bb);
+      float o0 = va, o1 = vb;
+      if (rot) {
+        o0 = __fsub_rn(__fmul_rn(va, cs), __fmul_rn(vb, sn));
+        o1 = __fadd_rn(__fmul_rn(va, sn), __fmul_rn(vb, cs));
+      }
+      if (warp == 0) {
+        sq[2 * lane] = bf16_round(o0);
+        sq[2 * lane + 1] = bf16_round(o1);
+      } else {
+        const uint32_t row = pack_bf16x2(o0, o1);
+        __nv_bfloat16* dst = kv_pool + ((layer_off + new_page) * 2 + (warp - 1)) * v_off + head_off + (cur & 63) * 64 + 2 * lane;
+        *reinterpret_cast<uint32_t*>(dst) = row;
+        *reinterpret_cast<uint32_t*>(&s_new[warp - 1][2 * lane]) = row;
+      }
+    }
+    __syncthreads();                                     // q, the new row and the ring's barriers visible to the block
+#pragma unroll
+    for (int j = 0; j < 8; ++j) qv[j] = sq[sub * 8 + j];
+  } else {
+    const uint4 qq = *reinterpret_cast<const uint4*>(q + (static_cast<long long>(seq) * n_heads + head) * 64 + sub * 8);
+    const uint32_t w[4] = {qq.x, qq.y, qq.z, qq.w};
+#pragma unroll
+    for (int j = 0; j < 4; ++j) { qv[2 * j] = bf16_lo(w[j]); qv[2 * j + 1] = bf16_hi(w[j]); }
+    __syncthreads();                                     // the ring's barriers initialised
+  }
+  if (tl) tl_s[2] = tl_now();
+  float m = -INFINITY, l = 0.f;
+  float acc[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) acc[j] = 0.f;
+
+  for (int k = 0; k < n_stages; ++k) {
+    mbar_wait(&full_bar[k % kDecStages], (k / kDecStages) & 1);
+    const uint4* sk = reinterpret_cast<const uint4*>(ring + (k % kDecStages) * kDecStageElems + warp * 8 * 64);
+    const uint4* sv = sk + 4 * 8 * 8;                   // the V plane: 4 warps x 8 rows x 8 chunks further
+    const int k0 = (k >> 1) * kPageTokens + warp * 16 + (k & 1) * 8;
+    uint4 kq[2], vq[2];
+#pragma unroll
+    for (int st = 0; st < 2; ++st) {
+      const int r = st * 4 + rowi;
+      const bool fresh = FUSED && k0 + r == cur;
+      kq[st] = fresh ? reinterpret_cast<const uint4*>(s_new[0])[sub] : sk[r * 8 + sub];
+      vq[st] = fresh ? reinterpret_cast<const uint4*>(s_new[1])[sub] : sv[r * 8 + sub];
+    }
+#pragma unroll
+    for (int st = 0; st < 2; ++st) {
+      const int kpos = k0 + st * 4 + rowi;
+      const uint32_t w[4] = {kq[st].x, kq[st].y, kq[st].z, kq[st].w};
+      float d = 0.f;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) d += qv[2 * j] * bf16_lo(w[j]) + qv[2 * j + 1] * bf16_hi(w[j]);
+      d += __shfl_xor_sync(0xffffffffu, d, 1);
+      d += __shfl_xor_sync(0xffffffffu, d, 2);
+      d += __shfl_xor_sync(0xffffffffu, d, 4);
+      if (kpos < kv_len) {               // uniform within the 8-lane group
+        const float sc = d * scale_log2;
+        const float mn = fmaxf(m, sc);
+        const float c = exp2f(m - mn);
+        const float pw = exp2f(sc - mn);
+        l = l * c + pw;
+        const uint32_t u[4] = {vq[st].x, vq[st].y, vq[st].z, vq[st].w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          acc[2 * j] = acc[2 * j] * c + pw * bf16_lo(u[j]);
+          acc[2 * j + 1] = acc[2 * j + 1] * c + pw * bf16_hi(u[j]);
+        }
+        m = mn;
+      }
+    }
+    __syncthreads();                                     // the stage is consumed: refill it
+    if (tid == 0 && k + kDecStages < n_stages) issue(k + kDecStages);
+  }
+
+  if (tl) tl_s[3] = tl_now();
+  // merge the 16 partial states as decode_attention_kernel does; the ring is idle now and holds them
+  float* sm_m = reinterpret_cast<float*>(dec_smem);      // [16][8]
+  float* sm_l = sm_m + 128;                              // [16][8]
+  float* sm_acc = sm_l + 128;                            // [16][8][8]
+  const int slot = warp * 4 + rowi;
+  sm_m[slot * 8 + sub] = m;
+  sm_l[slot * 8 + sub] = l;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) sm_acc[(slot * 8 + sub) * 8 + j] = acc[j];
+  __syncthreads();
+  if (tid < 64) {
+    const int c = tid >> 3, j = tid & 7;
+    float M = -INFINITY;
+#pragma unroll
+    for (int s2 = 0; s2 < 16; ++s2) M = fmaxf(M, sm_m[s2 * 8 + c]);
+    float L = 0.f, A = 0.f;
+#pragma unroll
+    for (int s2 = 0; s2 < 16; ++s2) {
+      const float w = (sm_m[s2 * 8 + c] == -INFINITY) ? 0.f : exp2f(sm_m[s2 * 8 + c] - M);
+      L += sm_l[s2 * 8 + c] * w;
+      A += sm_acc[(s2 * 8 + c) * 8 + j] * w;
+    }
+    out[static_cast<long long>(seq) * ld_out + head * 64 + c * 8 + j] = __float2bfloat16_rn(A / L);
+  }
+  if (tl) tl_emit((2u << 28) | (FUSED ? 1u : 0u), tl_s[0], tl_s[1], tl_s[2], tl_s[3], tl_now());
+}
+
 void timeline_install_attention(const Timeline& t) { timeline_install(t); }
+
+template <bool FUSED>
+static int launch_decode_attention(const __nv_bfloat16* q, int n_heads, int n_kv_heads, const int* pos, int n_seqs,
+                                   __nv_bfloat16* kv_pool, int n_pages, const int* block_tables, int max_blocks,
+                                   int layer, __nv_bfloat16* out, long long ld_out, const DecodeFuse& fz,
+                                   cudaStream_t stream) {
+  const float scale_log2 = 0.125f * 1.4426950408889634f;
+  const dim3 grid(n_heads, n_seqs);
+  count_launch();
+  const cudaError_t e =
+      g_attention_impl == 2
+          ? launch_k(decode_attention_kernel<FUSED>, grid, dim3(128), 0, stream, q, n_heads, n_kv_heads, pos, kv_pool,
+                     n_pages, block_tables, max_blocks, layer, out, ld_out, scale_log2, fz)
+          : launch_k(decode_attention_ring_kernel<FUSED>, grid, dim3(128), kDecSmem, stream, q, n_heads, n_kv_heads,
+                     pos, kv_pool, n_pages, block_tables, max_blocks, layer, out, ld_out, scale_log2, fz);
+  if (e != cudaSuccess) return set_error(cudaGetErrorString(e));
+  return 0;
+}
 
 int decode_attention(const __nv_bfloat16* q, int n_heads, int n_kv_heads, const int* pos, int n_seqs,
                      const __nv_bfloat16* kv_pool, int n_pages, const int* block_tables,
@@ -546,13 +784,8 @@ int decode_attention(const __nv_bfloat16* q, int n_heads, int n_kv_heads, const 
   if (n_seqs <= 0) return set_error("decode_attention: empty batch");
   if (n_kv_heads <= 0) n_kv_heads = n_heads;
   if (n_heads % n_kv_heads) return set_error("decode_attention: n_heads must be a multiple of n_kv_heads");
-  dim3 grid(n_heads, n_seqs);
-  count_launch();
-  cudaError_t e = launch_k(decode_attention_kernel<false>, grid, dim3(128), 0, stream, q, n_heads, n_kv_heads, pos,
-                           const_cast<__nv_bfloat16*>(kv_pool), n_pages, block_tables, max_blocks, layer, out, ld_out,
-                           0.125f * 1.4426950408889634f, DecodeFuse{});
-  if (e != cudaSuccess) return set_error(cudaGetErrorString(e));
-  return 0;
+  return launch_decode_attention<false>(q, n_heads, n_kv_heads, pos, n_seqs, const_cast<__nv_bfloat16*>(kv_pool),
+                                        n_pages, block_tables, max_blocks, layer, out, ld_out, DecodeFuse{}, stream);
 }
 
 // fused form: q/k/v/fc1 are finished from the split-K partials `ws` inside the kernel (see DecodeFuse)
@@ -563,13 +796,8 @@ int decode_attention_fused(const float* ws, int splits, int D, int FF, const __n
   if (n_seqs <= 0) return set_error("decode_attention: empty batch");
   if (FF % n_heads || (FF / n_heads) % 2) return set_error("decode_attention_fused: FF must split evenly over the heads");
   DecodeFuse fz{ws, splits, n_seqs, D, FF, bias, freqs, hid, ld_hid};
-  dim3 grid(n_heads, n_seqs);
-  count_launch();
-  cudaError_t e = launch_k(decode_attention_kernel<true>, grid, dim3(128), 0, stream,
-                           static_cast<const __nv_bfloat16*>(nullptr), n_heads, n_heads, pos, kv_pool, n_pages, block_tables,
-                           max_blocks, layer, out, ld_out, 0.125f * 1.4426950408889634f, fz);
-  if (e != cudaSuccess) return set_error(cudaGetErrorString(e));
-  return 0;
+  return launch_decode_attention<true>(static_cast<const __nv_bfloat16*>(nullptr), n_heads, n_heads, pos, n_seqs,
+                                       kv_pool, n_pages, block_tables, max_blocks, layer, out, ld_out, fz, stream);
 }
 
 // ------------------------------------------------------------------------------------------------

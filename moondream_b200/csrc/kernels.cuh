@@ -177,7 +177,9 @@ int prefill_attention_tc(const __nv_bfloat16* q, int n_heads, int n_kv_heads, in
                          int max_blocks, int layer, __nv_bfloat16* out, cudaStream_t stream);
 int vit_attention_tc(const __nv_bfloat16* qkv, int n_crops, int seq, int n_heads, __nv_bfloat16* out,
                      cudaStream_t stream);
-extern int g_attention_impl;   // 1: the mma.sync kernels of attention.cu; otherwise the wgmma kernels
+// 1: the mma.sync kernels of attention.cu; otherwise the wgmma kernels.  Decode attention: 2 = the kernel that loads
+// K/V into registers instead of the bulk-copy ring (same bits).
+extern int g_attention_impl;
 
 // ---- attention.cu ----
 int vit_attention(const __nv_bfloat16* qkv, int n_crops, int seq, int n_heads, __nv_bfloat16* out,

@@ -91,6 +91,14 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* t
       : "memory");
 }
 
+// 1-D bulk copy of `bytes` (a multiple of 16, both addresses 16-byte aligned) global -> this CTA's shared memory
+__device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
+  asm volatile(
+      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(smem_dst)),
+      "l"(reinterpret_cast<uint64_t>(gsrc)), "r"(bytes), "r"(smem_u32(bar))
+      : "memory");
+}
+
 // 3-D tiled load (c0 innermost)
 __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* tm, uint64_t* bar,
                                             int32_t c0, int32_t c1, int32_t c2) {
