@@ -219,17 +219,20 @@ def test_patchify_is_bit_exact(n_crops):
     assert bool((out[:, C * P * P:] == 0).all())
 
 
-@pytest.mark.parametrize("tilings", [[(1, 1)], [(2, 2), (1, 1), (3, 3)], [(1, 2), (3, 4), (2, 1)]])
-def test_stitch_pool_concat_matches_the_reference_ops(tilings):
+@pytest.mark.parametrize("tilings", [[(1, 1)], [(2, 2), (1, 1), (3, 3)], [(1, 2), (3, 4), (2, 1)],
+                                     [(1, 9), (2, 6), (9, 1)], [(6, 2), (1, 1), (1, 9)]])
+@pytest.mark.parametrize("dim", [144, 720, 1152])
+def test_stitch_pool_concat_matches_the_reference_ops(dim, tilings):
     """reconstruct_from_crops(patch_size = 1) + adaptive_avg_pool2d + concat (image_crops.py:170-231, vision.py:83-88)
     against the oracle's restatement run with torch CPU bf16 ops: bit-exact (fp32 window sums in row-major order,
-    divided by the count, like ATen)."""
+    divided by the count, like ATen).  (1, 9) and (9, 1) stitch 27 x 179 and 179 x 27 maps, whose pool windows
+    are uneven and overlap; the widths are the tiny, 0.5B and 2B encoders'."""
     import torch.nn.functional as F
 
     from oracle.moondream_oracle import stitch_crops
 
     N, lib = _lib()
-    g, margin, dim = 27, 4, 144
+    g, margin = 27, 4
     n_crops = [1 + th * tw for th, tw in tilings]
     offs = [0]
     for c in n_crops:
